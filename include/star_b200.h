@@ -334,6 +334,32 @@ int star_gpu_sa_build(int device, const uint8_t* G, uint64_t nGenome, uint32_t G
  * shards) and <dir>Log.final.out; dir = <shard prefix>_STARpass1/. */
 int star_host_merge_pass1(int argc, char** argv, int nShards, const char* dir);
 
+/* ---- signal tracks (--outWigType, --runMode inputAlignmentsFromBAM; reference source/signalFromBAM.cpp:5-209) ------------------------
+ * The host decodes the BAM records of one segment (a run of records with the same reference, signalFromBAM.cpp:78-120) into blocks in
+ * record order; the device builds the per-base tracks of the segment and returns only the positions where a track's output changes.
+ * Track t = 2*strand + k: k = 0 "Unique" (number of NH==1 records covering the base), k = 1 "UniqueMultiple" (left fold, in record order,
+ * of 1.0/NH over the records covering the base, as the reference's `sigAll[..] += 1.0/aNH` sums it).  All pointers are HOST pointers. */
+typedef struct star_signal_block {
+    uint32_t start;   /* first position (0-based) of the segment this record adds to */
+    uint32_t len;     /* positions start .. start+len-1 (start+len <= chrLen) */
+    uint32_t nh;      /* NH of the record, >= 1 */
+    uint32_t strand;  /* 0 or 1; always 0 for an unstranded run */
+} star_signal_block_t;
+typedef struct star_signal_track {
+    const uint32_t* pos;   /* positions (0-based, increasing) ... */
+    const double* val;     /* ... and the track's value there (owned by the handle; valid until its next call) */
+    uint64_t n;
+} star_signal_track_t;
+typedef struct star_signal star_signal_t;
+/* nStrands = 1 (2 tracks) or 2 (4 tracks) */
+int star_gpu_signal_open(star_signal_t** h, int device, uint32_t nStrands);
+/* One segment of chrLen positions.  mode 0 (bedGraph): every position whose value differs from the position before (0 before position 0);
+ * mode 1 (wiggle): every position with a nonzero value.  tracks: 2*nStrands entries.  ms (may be NULL) receives the device time of the
+ * call's kernels (CUDA events).  Returns 0 or a STAR_EXIT_* code. */
+int star_gpu_signal_segment(star_signal_t* h, uint32_t chrLen, const star_signal_block_t* blocks, uint64_t nBlocks, int mode,
+                            star_signal_track_t* tracks, float* ms);
+void star_gpu_signal_close(star_signal_t* h);
+
 /* Engine indirection used by star_cli_main; tests drive the same host code with the CPU oracle. */
 typedef struct star_engine_vtbl {
     int (*init)(void** ctx, int device, const star_index_view_t*, const star_params_t*, uint32_t maxReads);
@@ -355,6 +381,10 @@ typedef struct star_engine_vtbl {
     void* (*host_alloc)(size_t bytes);
     void (*host_free)(void* p);
     int (*download_results)(void* ctx, star_align_batch_t* out);
+    /* signal tracks (same meaning as star_gpu_signal_*) */
+    int (*signal_open)(void** h, int device, uint32_t nStrands);
+    int (*signal_segment)(void* h, uint32_t chrLen, const star_signal_block_t* blocks, uint64_t nBlocks, int mode, star_signal_track_t* tracks, float* ms);
+    void (*signal_close)(void* h);
 } star_engine_vtbl_t;
 int star_cli_main_engine(int argc, char** argv, const star_engine_vtbl_t* engine);
 

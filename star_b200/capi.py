@@ -85,6 +85,13 @@ RESULT_DTYPE = np.dtype({
 })
 
 
+class SignalTrack(C.Structure):
+    _fields_ = [("pos", C.POINTER(C.c_uint32)), ("val", C.POINTER(C.c_double)), ("n", C.c_uint64)]
+
+
+SIGNAL_BLOCK_DTYPE = np.dtype([("start", "<u4"), ("len", "<u4"), ("nh", "<u4"), ("strand", "<u4")])   # star_signal_block_t
+
+
 def load_library(path=LIB_PATH):
     if not os.path.exists(path):
         raise ImportError("star_b200: %s is missing; run `python -c 'import __graft_entry__ as g; g.build()'` (or `make`) first — "
@@ -113,7 +120,43 @@ def load_library(path=LIB_PATH):
     lib.star_host_last_error.restype = C.c_char_p
     lib.star_cli_main.argtypes = [C.c_int, C.POINTER(C.c_char_p)]
     lib.star_cli_main.restype = C.c_int
+    lib.star_gpu_signal_open.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_uint32]
+    lib.star_gpu_signal_open.restype = C.c_int
+    lib.star_gpu_signal_segment.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_int, C.POINTER(SignalTrack), C.POINTER(C.c_float)]
+    lib.star_gpu_signal_segment.restype = C.c_int
+    lib.star_gpu_signal_close.argtypes = [C.c_void_p]
+    lib.star_gpu_signal_close.restype = None
     return lib
+
+
+class Signal:
+    """star_gpu_signal_open / _segment / _close: the per-base tracks of one segment from its blocks (SIGNAL_BLOCK_DTYPE, record order)."""
+
+    def __init__(self, lib, n_strands, device=0):
+        self.lib = lib
+        self.n_tracks = 2 * n_strands
+        h = C.c_void_p()
+        rc = lib.star_gpu_signal_open(C.byref(h), device, n_strands)
+        if rc:
+            raise StarError(rc, lib.star_gpu_last_error().decode())
+        self.h = h
+
+    def segment(self, chr_len, blocks, mode=0):
+        """mode 0 (bedGraph): positions where a track changes; 1 (wiggle): nonzero positions.  Returns [(pos, val)] per track, device ms."""
+        blocks = np.ascontiguousarray(blocks, dtype=SIGNAL_BLOCK_DTYPE)
+        tr = (SignalTrack * 4)()
+        ms = C.c_float()
+        rc = self.lib.star_gpu_signal_segment(self.h, chr_len, blocks.ctypes.data, len(blocks), mode, tr, C.byref(ms))
+        if rc:
+            raise StarError(rc, self.lib.star_gpu_last_error().decode())
+        out = [(np.ctypeslib.as_array(t.pos, (t.n,)).copy(), np.ctypeslib.as_array(t.val, (t.n,)).copy()) if t.n else
+               (np.zeros(0, np.uint32), np.zeros(0)) for t in tr[:self.n_tracks]]
+        return out, ms.value
+
+    def close(self):
+        if self.h:
+            self.lib.star_gpu_signal_close(self.h)
+            self.h = None
 
 
 class StarError(RuntimeError):

@@ -962,8 +962,13 @@ static int vt_sjdb_merge(void* h, const uint64_t* indSorted, uint64_t nInd, uint
 static int vt_set_sj_novel(void* c, const uint64_t* a, const uint64_t* b, uint64_t n) { return star_gpu_set_sj_novel((star_ctx_t*)c, a, b, n); }
 static void vt_sjdb_close(void* h) { star_gpu_sjdb_close((star_sjdb_t*)h); }
 static int vt_download(void* ctx, star_align_batch_t* out) { return star_gpu_download_results((star_ctx_t*)ctx, out); }
+static int vt_signal_open(void** h, int device, uint32_t nStrands) { return star_gpu_signal_open((star_signal_t**)h, device, nStrands); }
+static int vt_signal_segment(void* h, uint32_t chrLen, const star_signal_block_t* b, uint64_t nB, int mode, star_signal_track_t* tr, float* ms) {
+    return star_gpu_signal_segment((star_signal_t*)h, chrLen, b, nB, mode, tr, ms);
+}
+static void vt_signal_close(void* h) { star_gpu_signal_close((star_signal_t*)h); }
 static const star_engine_vtbl_t g_cuda_engine = {vt_init, vt_map, vt_destroy, star_gpu_last_error, vt_sjdb_open, vt_sjdb_search, vt_sjdb_merge, vt_sjdb_close, star_gpu_sa_build, vt_set_sj_novel,
-                                                 star_gpu_host_alloc, star_gpu_host_free, vt_download};
+                                                 star_gpu_host_alloc, star_gpu_host_free, vt_download, vt_signal_open, vt_signal_segment, vt_signal_close};
 
 int star_cli_main(int argc, char** argv) { return star_cli_main_engine(argc, argv, &g_cuda_engine); }
 

@@ -621,6 +621,17 @@ static int runAlign(int argc, char** argv, const star_engine_vtbl_t* eng) {
     for (const std::string& ip : P.ignoredParams) logMain << "star-b200: --" << ip << " is accepted and has no effect (no host-side buffer / temporary-file limits)\n";
     *g_logStd << "\t" << P.commandLine << "\n\tSTAR version: 2.7.11b (star-b200)\n" << timeMonthDayTime(stats.timeStart) << " ..... started STAR run\n" << std::flush;
 
+    if (P.runMode == "inputAlignmentsFromBAM") {   // Parameters.cpp:585-607
+        time_t t; time(&t);
+        *g_logStd << timeMonthDayTime(t) << " ..... reading from BAM, output wiggle\n" << std::flush;
+        logMain << timeMonthDayTime(t) << " ..... reading from BAM, output wiggle\n" << std::flush;
+        rc = signalFromBAMfile(P, eng, logMain, err);
+        if (rc) return exitWithError(err, rc, &logMain);
+        time(&t);
+        *g_logStd << timeMonthDayTime(t) << " ..... done\n" << std::flush;
+        logMain << timeMonthDayTime(t) << " ..... done\n" << std::flush;
+        return 0;
+    }
     if (P.runMode == "genomeGenerate") {   // STAR.cpp:120-125
         rc = genomeGenerate(P, eng, logMain, err);
         if (rc) return exitWithError(err, rc, &logMain);
@@ -770,6 +781,17 @@ static int runAlign(int argc, char** argv, const star_engine_vtbl_t* eng) {
         time_t tFinishMap; time(&tFinishMap);
         *g_logStd << timeMonthDayTime(tFinishMap) << " ..... finished mapping\n" << std::flush;
         logMain << timeMonthDayTime(tFinishMap) << " ..... finished mapping\n";
+    }
+    if (P.wigYes && P.gpuShardCount == 1) {   // STAR.cpp:274-283, from the sorted records still in memory (sharded runs: star_b200.dist after the merge)
+        time_t t; time(&t);
+        *g_logStd << timeMonthDayTime(t) << " ..... started wiggle output\n" << std::flush;
+        logMain << timeMonthDayTime(t) << " ..... started wiggle output\n" << std::flush;
+        std::vector<const uint8_t*> recs(stage.coordIndex.size());
+        for (size_t i = 0; i < recs.size(); i++) recs[i] = (const uint8_t*)stage.coordBlobs[stage.coordIndex[i].blob].data() + stage.coordIndex[i].off;
+        std::vector<uint32_t> lens(idx.chrName.size());
+        for (size_t i = 0; i < lens.size(); i++) lens[i] = (uint32_t)idx.view.chrLength[i];
+        rc = signalFromRecords(P, eng, idx.chrName, lens, recs, logMain, err);
+        if (rc) return exitWithError(err, rc, &logMain);
     }
     time(&stats.timeFinish);
     if (stage.geneModel) stage.geneCounts.write(geneModel, stats, P.outFileNamePrefix + "ReadsPerGene.out.tab");   // STAR.cpp:258-265 (a shard: its part)

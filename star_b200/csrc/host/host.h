@@ -120,6 +120,12 @@ struct HostParams {
     uint64_t twopass1readsN = ~0ULL;
     bool twoPassYes = false, sjdbInsertPass1 = false, sjdbInsertPass2 = false, sjdbInsertYes = false;
     std::string twoPassDir, sjdbInsertOutDir;
+    // signal tracks (Parameters.cpp:511-562, 585-607, 685-690): --outWigType bedGraph|wiggle [read1_5p|read2], after the coordinate sort of
+    // a mapping run or from --inputBAMfile with --runMode inputAlignmentsFromBAM
+    std::vector<std::string> outWigType = {"None"}, outWigStrand = {"Stranded"}, outWigNorm = {"RPM"};
+    std::string outWigReferencesPrefix = "-", inputBAMfile = "-";
+    bool wigYes = false, wigStranded = true;
+    int wigFormat = 0, wigType = 0, wigNorm = 1;   // format 0 bedGraph / 1 wiggle; type 0 all M bases / 1 read1_5p / 2 read2; norm 0 None / 1 RPM
     // star-b200 extensions (not in the reference)
     int gpuDevice = 0;
     unsigned gpuChunkReads = 65536;         // reads (pairs) per engine call (3 chunks are in flight); larger contexts do not fit an 80 GB H100 beside a GRCh38-sized index
@@ -167,6 +173,13 @@ int genomeGenerate(HostParams& P, const star_engine_vtbl_t* eng, std::ostream& l
 int sjdbInsertJunctions(const HostParams& P, star_params_t* hp, LoadedIndex& idx, SjdbLoci& loci, bool pass2, const std::string& pass1sjFile,
                         const star_engine_vtbl_t* eng, std::ostream& logMain, std::string& err, bool generateMode = false);
 int loadIndex(const std::string& genomeDir, star_params_t* p, LoadedIndex& L, std::string& err, std::string* log, bool chrInfoOnly = false);
+
+// ---- signal tracks (signal.cpp; signalFromBAM.cpp:5-209): <prefix>Signal.{Unique,UniqueMultiple}.str{1,2}.out.{bg,wig} ----------------
+// recs: the BAM records in file order, each pointing at its block_size field; names / lens: the references of the header.
+int signalFromRecords(const HostParams& P, const star_engine_vtbl_t* eng, const std::vector<std::string>& names, const std::vector<uint32_t>& lens,
+                      const std::vector<const uint8_t*>& recs, std::ostream& logMain, std::string& err);
+// --runMode inputAlignmentsFromBAM: reads --inputBAMfile (BGZF, inflated on the host stage threads)
+int signalFromBAMfile(const HostParams& P, const star_engine_vtbl_t* eng, std::ostream& logMain, std::string& err);
 
 // one chunk of reads in host memory
 struct ReadChunk {

@@ -117,7 +117,7 @@ bool parseU64(const std::string& s, uint64_t& out) {
 const char* kUnsupported[] = {
     "genomeChainFiles", "genomeFileSizes", "genomeTransformOutput", "genomeChrSetMitochondrial", "genomeSuffixLengthMax",
     "genomeTransformType", "genomeTransformVCF", "genomeType", "varVCFfile", "readFilesType", "readFilesSAMattrKeep", "outSAMfilter",
-    "outWigType", "outWigStrand", "outWigReferencesPrefix", "outWigNorm", "peOverlapNbasesMin", "peOverlapMMp", "chimOutType",
+    "bamRemoveDuplicatesType", "bamRemoveDuplicatesMate2basesN", "peOverlapNbasesMin", "peOverlapMMp", "chimOutType",
     "chimSegmentMin", "chimScoreMin", "chimScoreDropMax", "chimScoreSeparation", "chimScoreJunctionNonGTAG", "chimJunctionOverhangMin",
     "chimSegmentReadGapMax", "chimFilter", "chimMainSegmentMultNmax", "chimMultimapNmax", "chimMultimapScoreRange",
     "chimNonchimScoreDropMin", "chimOutJunctionFormat", "waspOutputMode", "soloType", "soloCBtype", "soloCBwhitelist", "soloCBstart",
@@ -210,6 +210,8 @@ int parseCommandLine(int argc, char** argv, HostParams& P, std::string& err) {
     STR("alignEndsType", &P.alignEndsType); VSTR("alignEndsProtrude", &P.alignEndsProtrude);
     STR("alignSoftClipAtReferenceEnds", &P.alignSoftClipAtReferenceEnds); STR("alignInsertionFlush", &P.alignInsertionFlush);
     STR("outMultimapperOrder", &P.outMultimapperOrder);
+    VSTR("outWigType", &P.outWigType); VSTR("outWigStrand", &P.outWigStrand); VSTR("outWigNorm", &P.outWigNorm);
+    STR("outWigReferencesPrefix", &P.outWigReferencesPrefix); STR("inputBAMfile", &P.inputBAMfile);
     tab["runThreadN"] = Setter{[&P](const Vals& v) { return v.size() == 1 && parseNum(v[0], P.runThreadN) && P.runThreadN > 0; }};
     tab["readMapNumber"] = Setter{[&P](const Vals& v) { return v.size() == 1 && parseNum(v[0], P.readMapNumber); }};
     tab["outSAMattrIHstart"] = Setter{[&P](const Vals& v) { return v.size() == 1 && parseNum(v[0], P.outSAMattrIHstart); }};
@@ -314,6 +316,26 @@ int parseCommandLine(int argc, char** argv, HostParams& P, std::string& err) {
 int finalizeParams(HostParams& P, std::string& err) {
     star_params_t& h = P.hp;
     auto bad = [&](const std::string& m) { err = m; return STAR_EXIT_PARAMETER; };
+    // Parameters.cpp:511-562
+    if (P.outWigType[0] == "None") P.wigYes = false;
+    else if (P.outWigType[0] == "bedGraph") { P.wigYes = true; P.wigFormat = 0; }
+    else if (P.outWigType[0] == "wiggle") { P.wigYes = true; P.wigFormat = 1; }
+    else return bad("EXITING because of FATAL INPUT ERROR: unrecognized option in --outWigType=" + P.outWigType[0] + "\nSOLUTION: use one of the allowed values of --outWigType : 'None' or 'bedGraph' \n");
+    if (P.outWigStrand[0] == "Stranded") P.wigStranded = true;
+    else if (P.outWigStrand[0] == "Unstranded") P.wigStranded = false;
+    else return bad("EXITING because of FATAL INPUT ERROR: unrecognized option in --outWigStrand=" + P.outWigStrand[0] + "\nSOLUTION: use one of the allowed values of --outWigStrand : 'Stranded' or 'Unstranded' \n");
+    if (P.outWigType.size() == 1) P.wigType = 0;
+    else if (P.outWigType[1] == "read1_5p") P.wigType = 1;
+    else if (P.outWigType[1] == "read2") P.wigType = 2;
+    else return bad("EXITING because of FATAL INPUT ERROR: unrecognized second option in --outWigType=" + P.outWigType[1] + "\nSOLUTION: use one of the allowed values of --outWigType : 'read1_5p' \n");
+    if (P.outWigNorm[0] == "None") P.wigNorm = 0;
+    else if (P.outWigNorm[0] == "RPM") P.wigNorm = 1;
+    else return bad("EXITING because of fatal parameter ERROR: unrecognized option in --outWigNorm=" + P.outWigNorm[0] + "\nSOLUTION: use one of the allowed values of --outWigNorm : 'None' or 'RPM' \n");
+    if (P.runMode == "inputAlignmentsFromBAM") {   // Parameters.cpp:585-607: no genome, no reads; --bamRemoveDuplicatesType is outside the scope
+        if (!P.wigYes)
+            return bad("EXITING because of fatal INPUT ERROR: at the moment --runMode inputFromBAM only works with --outWigType bedGraph OR --bamRemoveDuplicatesType Identical\n");
+        return 0;
+    }
     if (P.runMode == "genomeGenerate") {   // index generation (genome_generate.cpp): only the genome / junction parameters matter
         if (P.genomeFastaFiles.empty() || P.genomeFastaFiles[0] == "-")
             return bad("EXITING because of fatal PARAMETERS error: --runMode genomeGenerate needs --genomeFastaFiles\n");
@@ -325,7 +347,7 @@ int finalizeParams(HostParams& P, std::string& err) {
         return 0;
     }
     if (P.runMode != "alignReads")
-        return bad("EXITING because of fatal input ERROR: star-b200 implements --runMode alignReads and genomeGenerate only\n");
+        return bad("EXITING because of fatal input ERROR: star-b200 implements --runMode alignReads, genomeGenerate and inputAlignmentsFromBAM only\n");
     if (P.genomeLoad == "LoadAndKeep" || P.genomeLoad == "LoadAndRemove") {   // the index lives in this process' HBM; nothing is shared or kept
         if (P.twopassMode != "None" || P.sjdbFileChrStartEnd[0] != "-" || P.sjdbGTFfile != "-")   // Parameters.cpp:809-814, 1012-1017
             return bad("EXITING because of fatal PARAMETERS error: on the fly junction insertion and 2-pass mappng cannot be used with shared memory genome \nSOLUTION: run STAR with --genomeLoad NoSharedMemory to avoid using shared memory\n");
@@ -475,6 +497,10 @@ int finalizeParams(HostParams& P, std::string& err) {
         }
     } else if (P.outSAMtype[0] != "SAM")
         return bad("EXITING because of fatal input ERROR: unknown value for the first word of outSAMtype: " + P.outSAMtype[0] + "\nSOLUTION: re-run STAR with one of the allowed values of outSAMtype: BAM or SAM \n");
+    if (!P.outBAMcoord && P.wigYes)   // Parameters.cpp:685-690
+        return bad("EXITING because of fatal PARAMETER error: generating signal with --outWigType requires sorted BAM\nSOLUTION: re-run STAR with with --outSAMtype BAM SortedByCoordinate, or, id you also need unsroted BAM, with --outSAMtype BAM SortedByCoordinate Unsorted\n");
+    if (P.wigYes && P.outStd == "BAM_SortedByCoordinate")   // (the reference would read the signal back from "-", i.e. standard input)
+        return bad("EXITING because of fatal PARAMETER error: --outWigType cannot be combined with --outStd BAM_SortedByCoordinate: the signal is made from the sorted BAM file\nSOLUTION: re-run STAR with --outStd Log, or make the signal from the BAM with --runMode inputAlignmentsFromBAM\n");
     if (P.outSAMmode != "Full" && P.outSAMmode != "NoQS" && P.outSAMmode != "None")
         return bad("EXITING because of FATAL input ERROR: unknown value for the option --outSAMmode=" + P.outSAMmode + "\nSOLUTION: use one of the allowed values: None or Full or NoQS\n");
     if (P.outSAMorder != "Paired" && P.outSAMorder != "PairedKeepInputOrder")   // (records are always written in input order, which both values allow)

@@ -47,6 +47,23 @@ def shard_args(argv, rank, world, device=None):
     return out
 
 
+def signal_args(argv, prefix):
+    """--outWigType of a sharded run: the command line that makes the tracks from the merged Aligned.sortedByCoord.out.bam (rank 0, after
+    the merge), or None.  The shards write no tracks: the reference builds them from the whole sorted BAM (STAR.cpp:274-283)."""
+    keep = ("outWigType", "outWigStrand", "outWigNorm", "outWigReferencesPrefix", "runThreadN", "gpuDevice")
+    groups, cur = [], None
+    for a in argv:
+        if a.startswith("--"):
+            cur = [a]
+            groups.append(cur)
+        elif cur is not None:
+            cur.append(a)
+    out = [x for g in groups if g[0][2:].split("=")[0] in keep for x in g]
+    if not any(x.startswith("--outWigType") for x in out) or "None" in [g[1] for g in groups if g[0] == "--outWigType" and len(g) > 1]:
+        return None
+    return ["--runMode", "inputAlignmentsFromBAM", "--inputBAMfile", prefix + "Aligned.sortedByCoord.out.bam", "--outFileNamePrefix", prefix] + out
+
+
 def read_shard_counters(prefix, rank):
     with open(prefix + "shard%d.shard.bin" % rank, "rb") as f:
         return np.frombuffer(f.read(8 * N_COUNTERS), dtype=np.uint64).copy()
@@ -211,6 +228,15 @@ def run_sharded(argv, cli=None, backend=None):
         arr = (C.c_char_p * len(margv))(*[a.encode() for a in margv])
         rc = lib.star_host_merge_shards(len(margv), arr, world, total.ctypes.data)
         _timed("merge_shards_s", t0)
+        sig = signal_args(argv, _prefix(argv))
+        if rc == 0 and sig is not None:   # the tracks of the whole run, once, from the merged sorted BAM
+            t0 = time.time()
+            if cli is None:
+                sarr = (C.c_char_p * (len(sig) + 1))(*([prog.encode()] + [x.encode() for x in sig]))
+                rc = lib.star_cli_main(len(sig) + 1, sarr)
+            else:
+                rc = subprocess.call([cli] + sig, stdout=subprocess.DEVNULL)
+            _timed("signal_s", t0)
         TIMING["total_s"] = time.time() - t_all
         TIMING["world"] = world
         try:
