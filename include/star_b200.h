@@ -360,6 +360,21 @@ int star_gpu_signal_segment(star_signal_t* h, uint32_t chrLen, const star_signal
                             star_signal_track_t* tracks, float* ms);
 void star_gpu_signal_close(star_signal_t* h);
 
+/* ---- duplicate marking (--bamRemoveDuplicatesType with --runMode inputAlignmentsFromBAM; reference source/bamRemoveDuplicates.cpp) ----
+ * The host marks the records and finds the groups; the device pairs the NH == 1 members of each group in name order, classes the pairs by
+ * start, flags, S-extended CIGARs and the compared mate-2 bases, and picks the pair of every class whose first record has the highest AS
+ * (ties: the first in name order).  All pointers are HOST pointers. */
+typedef struct star_dedup star_dedup_t;
+int star_gpu_dedup_open(star_dedup_t** h, int device, uint64_t mate2basesN);
+/* n members in file order: member i's record (its block_size field) is at bytes + offsets[i] (offsets increasing), groups[i] its group
+ * (non-decreasing; a batch holds whole groups).  unmark[i] (n bytes) receives 1 for every record of a winning pair, else 0.  ms (may be
+ * NULL) receives the device time (CUDA events).  Returns 0, or STAR_EXIT_INPUT_FILES (a record the reference cannot compare: a CIGAR
+ * without 1..100 operations that are not all S, fewer bases than mate2basesN, malformed optional fields, AS <= -999) or
+ * STAR_EXIT_PARAMETER (AS missing) with unmark[] all 0 except 2 + kind at the member named (kind 0 CIGAR, 1 bases, 2 optional fields,
+ * 3 AS missing, 4 AS <= -999): the first such member of the first group that has one. */
+int star_gpu_dedup_batch(star_dedup_t* h, const uint8_t* bytes, const uint64_t* offsets, const uint32_t* groups, uint64_t n, uint8_t* unmark, float* ms);
+void star_gpu_dedup_close(star_dedup_t* h);
+
 /* Engine indirection used by star_cli_main; tests drive the same host code with the CPU oracle. */
 typedef struct star_engine_vtbl {
     int (*init)(void** ctx, int device, const star_index_view_t*, const star_params_t*, uint32_t maxReads);
@@ -385,6 +400,10 @@ typedef struct star_engine_vtbl {
     int (*signal_open)(void** h, int device, uint32_t nStrands);
     int (*signal_segment)(void* h, uint32_t chrLen, const star_signal_block_t* blocks, uint64_t nBlocks, int mode, star_signal_track_t* tracks, float* ms);
     void (*signal_close)(void* h);
+    /* duplicate marking (same meaning as star_gpu_dedup_*); may be NULL */
+    int (*dedup_open)(void** h, int device, uint64_t mate2basesN);
+    int (*dedup_batch)(void* h, const uint8_t* bytes, const uint64_t* offsets, const uint32_t* groups, uint64_t n, uint8_t* unmark, float* ms);
+    void (*dedup_close)(void* h);
 } star_engine_vtbl_t;
 int star_cli_main_engine(int argc, char** argv, const star_engine_vtbl_t* engine);
 

@@ -126,6 +126,12 @@ def load_library(path=LIB_PATH):
     lib.star_gpu_signal_segment.restype = C.c_int
     lib.star_gpu_signal_close.argtypes = [C.c_void_p]
     lib.star_gpu_signal_close.restype = None
+    lib.star_gpu_dedup_open.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_uint64]
+    lib.star_gpu_dedup_open.restype = C.c_int
+    lib.star_gpu_dedup_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(C.c_float)]
+    lib.star_gpu_dedup_batch.restype = C.c_int
+    lib.star_gpu_dedup_close.argtypes = [C.c_void_p]
+    lib.star_gpu_dedup_close.restype = None
     return lib
 
 
@@ -156,6 +162,37 @@ class Signal:
     def close(self):
         if self.h:
             self.lib.star_gpu_signal_close(self.h)
+            self.h = None
+
+
+class Dedup:
+    """star_gpu_dedup_open / _batch / _close: the pairs to un-mark among the NH == 1 members of whole groups (bamRemoveDuplicates)."""
+
+    def __init__(self, lib, mate2_bases_n=0, device=0):
+        self.lib = lib
+        h = C.c_void_p()
+        rc = lib.star_gpu_dedup_open(C.byref(h), device, mate2_bases_n)
+        if rc:
+            raise StarError(rc, lib.star_gpu_last_error().decode())
+        self.h = h
+
+    def batch(self, data, offsets, groups):
+        """data: the record bytes (uint8); offsets: uint64 offset of every member's record in data (increasing); groups: uint32 group of
+        every member (non-decreasing).  Returns (rc, unmark uint8 per member, device ms); rc != 0 is an input error, and unmark then holds
+        2 + kind at the member it names (include/star_b200.h)."""
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+        groups = np.ascontiguousarray(groups, dtype=np.uint32)
+        unmark = np.zeros(len(offsets), np.uint8)
+        ms = C.c_float()
+        rc = self.lib.star_gpu_dedup_batch(self.h, data.ctypes.data, offsets.ctypes.data, groups.ctypes.data, len(offsets), unmark.ctypes.data, C.byref(ms))
+        if rc not in (0, 102, 104):
+            raise StarError(rc, self.lib.star_gpu_last_error().decode())
+        return rc, unmark, ms.value
+
+    def close(self):
+        if self.h:
+            self.lib.star_gpu_dedup_close(self.h)
             self.h = None
 
 

@@ -967,8 +967,14 @@ static int vt_signal_segment(void* h, uint32_t chrLen, const star_signal_block_t
     return star_gpu_signal_segment((star_signal_t*)h, chrLen, b, nB, mode, tr, ms);
 }
 static void vt_signal_close(void* h) { star_gpu_signal_close((star_signal_t*)h); }
+static int vt_dedup_open(void** h, int device, uint64_t n2) { return star_gpu_dedup_open((star_dedup_t**)h, device, n2); }
+static int vt_dedup_batch(void* h, const uint8_t* bytes, const uint64_t* off, const uint32_t* grp, uint64_t n, uint8_t* unmark, float* ms) {
+    return star_gpu_dedup_batch((star_dedup_t*)h, bytes, off, grp, n, unmark, ms);
+}
+static void vt_dedup_close(void* h) { star_gpu_dedup_close((star_dedup_t*)h); }
 static const star_engine_vtbl_t g_cuda_engine = {vt_init, vt_map, vt_destroy, star_gpu_last_error, vt_sjdb_open, vt_sjdb_search, vt_sjdb_merge, vt_sjdb_close, star_gpu_sa_build, vt_set_sj_novel,
-                                                 star_gpu_host_alloc, star_gpu_host_free, vt_download, vt_signal_open, vt_signal_segment, vt_signal_close};
+                                                 star_gpu_host_alloc, star_gpu_host_free, vt_download, vt_signal_open, vt_signal_segment, vt_signal_close,
+                                                 vt_dedup_open, vt_dedup_batch, vt_dedup_close};
 
 int star_cli_main(int argc, char** argv) { return star_cli_main_engine(argc, argv, &g_cuda_engine); }
 

@@ -10,6 +10,7 @@
 #include <cstdio>
 #include <map>
 #include <cstdlib>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -126,6 +127,10 @@ struct HostParams {
     std::string outWigReferencesPrefix = "-", inputBAMfile = "-";
     bool wigYes = false, wigStranded = true;
     int wigFormat = 0, wigType = 0, wigNorm = 1;   // format 0 bedGraph / 1 wiggle; type 0 all M bases / 1 read1_5p / 2 read2; norm 0 None / 1 RPM
+    // duplicate marking (Parameters.cpp:566-580; --runMode inputAlignmentsFromBAM only): -> <prefix>Processed.out.bam
+    std::string bamRemoveDuplicatesType = "-";
+    uint64_t bamRemoveDuplicatesMate2basesN = 0;
+    bool dedupYes = false, dedupMarkMulti = false;
     // star-b200 extensions (not in the reference)
     int gpuDevice = 0;
     unsigned gpuChunkReads = 65536;         // reads (pairs) per engine call (3 chunks are in flight); larger contexts do not fit an 80 GB H100 beside a GRCh38-sized index
@@ -180,6 +185,15 @@ int signalFromRecords(const HostParams& P, const star_engine_vtbl_t* eng, const 
                       const std::vector<const uint8_t*>& recs, std::ostream& logMain, std::string& err);
 // --runMode inputAlignmentsFromBAM: reads --inputBAMfile (BGZF, inflated on the host stage threads)
 int signalFromBAMfile(const HostParams& P, const star_engine_vtbl_t* eng, std::ostream& logMain, std::string& err);
+// reads --inputBAMfile into u (inflated on the host stage threads): the header's references, recs = the records in file order (each at its
+// block_size field, inside u), headerEnd = the size of the header in u.  Returns 0 or STAR_EXIT_INPUT_FILES with the message in err.
+int readBAMfile(const HostParams& P, std::string& u, std::vector<std::string>& names, std::vector<uint32_t>& lens, std::vector<const uint8_t*>& recs,
+                size_t& headerEnd, std::string& err);
+// htslib bam_aux_get + bam_aux2i of the NH tag (has = false when there is none); false: malformed optional fields
+bool auxNH(const uint8_t* rec, bool& has, uint32_t& nh);
+void parallelFor(int n, int nT, const std::function<void(int)>& fn);
+// ---- duplicate marking (dedup.cpp; bamRemoveDuplicates.cpp:114-271): --inputBAMfile -> <prefix>Processed.out.bam
+int dedupFromBAMfile(const HostParams& P, const star_engine_vtbl_t* eng, std::ostream& logMain, std::string& err);
 
 // one chunk of reads in host memory
 struct ReadChunk {

@@ -19,9 +19,9 @@
 namespace starhost {
 
 namespace {
-
 inline uint32_t rd32(const uint8_t* p) { uint32_t v; memcpy(&v, p, 4); return v; }
 inline uint16_t rd16(const uint8_t* p) { uint16_t v; memcpy(&v, p, 2); return v; }
+}  // namespace
 
 // bam_aux_get + bam_aux2i (htslib sam.c): NH of the record; 0 = no NH tag (then *has = false).  A non-integer type reads as 0.
 bool auxNH(const uint8_t* rec, bool& has, uint32_t& nh) {
@@ -78,6 +78,7 @@ void parallelFor(int n, int nT, const std::function<void(int)>& fn) {
     for (auto& t : th) t.join();
 }
 
+namespace {
 struct Fmt {   // the number formatting of the output streams: fixed / precision 5 with RPM, default otherwise (libstdc++ formats via printf)
     bool rpm;
     void num(std::string& o, double v) const {
@@ -243,7 +244,8 @@ int signalFromRecords(const HostParams& P, const star_engine_vtbl_t* eng, const 
 
 // --inputBAMfile: BGZF blocks (htslib bgzf.c) indexed on one thread, inflated on the stage threads into one buffer, then the BAM header and
 // the record boundaries
-int signalFromBAMfile(const HostParams& P, const star_engine_vtbl_t* eng, std::ostream& logMain, std::string& err) {
+int readBAMfile(const HostParams& P, std::string& u, std::vector<std::string>& names, std::vector<uint32_t>& lens, std::vector<const uint8_t*>& recs,
+                size_t& headerEnd, std::string& err) {
     const std::string& fn = P.inputBAMfile;
     std::ifstream in(fn, std::ios::binary);
     if (!in.good()) { err = "EXITING because of fatal INPUT ERROR: could not open --inputBAMfile " + fn + "\nSOLUTION: check the path and permissions\n"; return STAR_EXIT_INPUT_FILES; }
@@ -270,7 +272,7 @@ int signalFromBAMfile(const HostParams& P, const star_engine_vtbl_t* eng, std::o
         uTot += uLen;
         o += bsize;
     }
-    std::string u(uTot, '\0');
+    u.assign(uTot, '\0');
     std::vector<char> okB(bl.size(), 1);
     const int nQ = P.stageThreads() * 4;
     parallelFor(nQ, P.stageThreads(), [&](int q) {
@@ -294,8 +296,8 @@ int signalFromBAMfile(const HostParams& P, const star_engine_vtbl_t* eng, std::o
     if (p + 4 > uTot) return bad("is truncated (in the header)");
     const uint32_t nRef = rd32(ub + p);
     p += 4;
-    std::vector<std::string> names(nRef);
-    std::vector<uint32_t> lens(nRef);
+    names.assign(nRef, std::string());
+    lens.assign(nRef, 0);
     for (uint32_t r = 0; r < nRef; r++) {
         if (p + 4 > uTot) return bad("is truncated (in the header)");
         const uint32_t ln = rd32(ub + p);
@@ -304,7 +306,8 @@ int signalFromBAMfile(const HostParams& P, const star_engine_vtbl_t* eng, std::o
         lens[r] = rd32(ub + p + 4 + ln);
         p += 8 + ln;
     }
-    std::vector<const uint8_t*> recs;
+    headerEnd = p;
+    recs.clear();
     while (p < uTot) {   // bam_read1: block_size, 32 bytes of fixed fields, then the variable part
         if (uTot - p < 4) return bad("is truncated (in a record)");
         const uint32_t bs = rd32(ub + p);
@@ -316,6 +319,16 @@ int signalFromBAMfile(const HostParams& P, const star_engine_vtbl_t* eng, std::o
         recs.push_back(r);
         p += 4 + (size_t)bs;
     }
+    return 0;
+}
+
+int signalFromBAMfile(const HostParams& P, const star_engine_vtbl_t* eng, std::ostream& logMain, std::string& err) {
+    std::string u;
+    std::vector<std::string> names;
+    std::vector<uint32_t> lens;
+    std::vector<const uint8_t*> recs;
+    size_t headerEnd = 0;
+    if (int rc = readBAMfile(P, u, names, lens, recs, headerEnd, err)) return rc;
     return signalFromRecords(P, eng, names, lens, recs, logMain, err);
 }
 
