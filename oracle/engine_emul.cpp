@@ -497,6 +497,13 @@ int engine_emul_seed_chunk(const star_index_view_t* view, const star_params_t* p
     return 0;
 }
 
+// The SA key of every row (build_sa_keys_kernel as one emulated CTA): keys[nSA].
+int engine_emul_sa_keys(const star_index_view_t* view, const star_params_t* params, uint32_t* keys) {
+    HostIndex hix(view, params);
+    runCta(256, [&] { build_sa_keys_kernel(hix.ix, keys); });
+    return 0;
+}
+
 int engine_emul_set_sj_novel(const uint64_t* sjStart, const uint64_t* sjEnd, uint64_t n) {
     if (n == ~0ULL) { g_sjNovelOn = false; return 0; }
     g_sjNovelStart.assign(sjStart, sjStart + n);
