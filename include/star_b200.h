@@ -375,6 +375,29 @@ int star_gpu_dedup_open(star_dedup_t** h, int device, uint64_t mate2basesN);
 int star_gpu_dedup_batch(star_dedup_t* h, const uint8_t* bytes, const uint64_t* offsets, const uint32_t* groups, uint64_t n, uint8_t* unmark, float* ms);
 void star_gpu_dedup_close(star_dedup_t* h);
 
+/* ---- adding references at the mapping stage (--genomeFastaFiles with --runMode alignReads; reference source/Genome_insertSequences.cpp,
+ * insertSeqSA.cpp) ------------------------------------------------------------------------------------------------------------------
+ * The host (star_b200/csrc/host/addref.cpp) scans the FASTA files, lays out the grown genome (the nG1 bytes of the added, padded
+ * chromosomes at nG = the old end of the chromosomes, the nG2 bytes of junction inserts moved behind them), sorts the insertion points and
+ * rebuilds SAindex; the steps that touch every SA row or every added suffix run on the GPU:
+ *   star_gpu_addref_open     uploads the grown G and the OLD SA and re-bases every old row in place (insertSeqSA.cpp:33-51): a forward row
+ *                            >= nG and a reverse row whose position is >= nG2 grow by nG1;
+ *   star_gpu_addref_search   for every suffix k of the 2*nG1-byte text (added sequences, then their reverse complement) the re-based row
+ *                            in front of which it goes: suffixArraySearch1(N = 10000, gInsert = nG, strR = k < nG1) (SuffixArrayFuns.cpp:210-351);
+ *   star_gpu_addref_merge_sa the new SA: inserted rows k + nG (forward) or (k - nG1 + nG2) | 1<<GstrandBit spliced in (insertSeqSA.cpp:158-199).
+ * ms (may be NULL) receives the device time of the call's kernel (CUDA events).  All pointers are HOST pointers. */
+typedef struct star_addref star_addref_t;
+/* grown: G = the grown genome (nGenome = nG + nG1 + nG2, 256 readable bytes of code 5 on both sides), SA / nSA / nSAbyte / GstrandBit = the
+ * OLD suffix array.  Fails with STAR_EXIT_MEMORY_ALLOCATION when G, the SA and the merged SA do not fit the free device memory. */
+int star_gpu_addref_open(star_addref_t** h, int device, const star_index_view_t* grown, uint64_t nG, uint64_t nG1, uint64_t nG2, float* ms);
+/* seq: 2*nG1 bytes, the added region forward then reverse complement.  indArray: 2 * (2*nG1) words; indArray[2k] = row ((uint64)-1: the
+ * suffix starts with a code > 3, (uint64)-2: behind the last row), indArray[2k+1] = k. */
+int star_gpu_addref_search(star_addref_t* h, const uint8_t* seq, uint64_t* indArray, float* ms);
+/* indSorted: nInd pairs (row, k) in insertion order.  SAnew receives nSAnewByte bytes = PackedArray of nSA + nInd rows.  Releases the
+ * device copy of G first (the merge does not read it); search cannot be called afterwards. */
+int star_gpu_addref_merge_sa(star_addref_t* h, const uint64_t* indSorted, uint64_t nInd, uint8_t* SAnew, uint64_t nSAnewByte, float* ms);
+void star_gpu_addref_close(star_addref_t* h);
+
 /* Engine indirection used by star_cli_main; tests drive the same host code with the CPU oracle. */
 typedef struct star_engine_vtbl {
     int (*init)(void** ctx, int device, const star_index_view_t*, const star_params_t*, uint32_t maxReads);
@@ -404,6 +427,11 @@ typedef struct star_engine_vtbl {
     int (*dedup_open)(void** h, int device, uint64_t mate2basesN);
     int (*dedup_batch)(void* h, const uint8_t* bytes, const uint64_t* offsets, const uint32_t* groups, uint64_t n, uint8_t* unmark, float* ms);
     void (*dedup_close)(void* h);
+    /* adding references (same meaning as star_gpu_addref_*) */
+    int (*addref_open)(void** h, int device, const star_index_view_t* grown, uint64_t nG, uint64_t nG1, uint64_t nG2, float* ms);
+    int (*addref_search)(void* h, const uint8_t* seq, uint64_t* indArray, float* ms);
+    int (*addref_merge_sa)(void* h, const uint64_t* indSorted, uint64_t nInd, uint8_t* SAnew, uint64_t nSAnewByte, float* ms);
+    void (*addref_close)(void* h);
 } star_engine_vtbl_t;
 int star_cli_main_engine(int argc, char** argv, const star_engine_vtbl_t* engine);
 

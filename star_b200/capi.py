@@ -196,6 +196,54 @@ class Dedup:
             self.h = None
 
 
+class AddRef:
+    """star_gpu_addref_open / _search / _merge_sa / _close: the device steps of adding references (include/star_b200.h).  prefix names
+    another library's functions with the same signatures (the CPU restatement and the emulated kernels of the tests)."""
+
+    def __init__(self, lib, view, nG, nG1, nG2, device=0, prefix="star_gpu_addref"):
+        self.lib, self.nG1, self.view = lib, nG1, view
+        self.f = {k: getattr(lib, prefix + "_" + k) for k in ("open", "search", "merge_sa", "close")}
+        self.f["open"].argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p]
+        self.f["search"].argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        self.f["merge_sa"].argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
+        self.f["close"].argtypes = [C.c_void_p]
+        self.f["close"].restype = None
+        h = C.c_void_p()
+        ms = C.c_float()
+        rc = self.f["open"](C.byref(h), device, C.addressof(view), nG, nG1, nG2, C.addressof(ms))
+        if rc:
+            raise StarError(rc, "addref open failed")
+        self.h, self.ms_open = h, ms.value
+
+    def search(self, text):
+        """text: the 2*nG1 bytes forward + reverse complement.  Returns (indArray uint64 [2*nG1, 2], device ms)."""
+        text = np.ascontiguousarray(text, dtype=np.uint8)
+        ind = np.zeros(4 * self.nG1 + 2, np.uint64)
+        ms = C.c_float()
+        rc = self.f["search"](self.h, text.ctypes.data, ind.ctypes.data, C.addressof(ms))
+        if rc:
+            raise StarError(rc, "addref search failed")
+        return ind[:4 * self.nG1].reshape(-1, 2), ms.value
+
+    def merge_sa(self, ind_sorted):
+        """ind_sorted: (nInd, 2) uint64 in insertion order.  Returns (the merged SA bytes, device ms)."""
+        ind_sorted = np.ascontiguousarray(ind_sorted, dtype=np.uint64)
+        nInd = len(ind_sorted)
+        nSAnew = self.view.nSA + nInd
+        nbyte = (nSAnew - 1) * (self.view.GstrandBit + 1) // 8 + 8
+        out = np.zeros(nbyte + 16, np.uint8)
+        ms = C.c_float()
+        rc = self.f["merge_sa"](self.h, ind_sorted.ctypes.data, nInd, out.ctypes.data, nbyte, C.addressof(ms))
+        if rc:
+            raise StarError(rc, "addref merge failed")
+        return out[:nbyte], ms.value
+
+    def close(self):
+        if self.h:
+            self.f["close"](self.h)
+            self.h = None
+
+
 class StarError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__("star_b200 error %d: %s" % (code, msg))

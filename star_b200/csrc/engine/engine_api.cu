@@ -972,9 +972,17 @@ static int vt_dedup_batch(void* h, const uint8_t* bytes, const uint64_t* off, co
     return star_gpu_dedup_batch((star_dedup_t*)h, bytes, off, grp, n, unmark, ms);
 }
 static void vt_dedup_close(void* h) { star_gpu_dedup_close((star_dedup_t*)h); }
+static int vt_addref_open(void** h, int device, const star_index_view_t* v, uint64_t nG, uint64_t nG1, uint64_t nG2, float* ms) {
+    return star_gpu_addref_open((star_addref_t**)h, device, v, nG, nG1, nG2, ms);
+}
+static int vt_addref_search(void* h, const uint8_t* seq, uint64_t* ind, float* ms) { return star_gpu_addref_search((star_addref_t*)h, seq, ind, ms); }
+static int vt_addref_merge(void* h, const uint64_t* ind, uint64_t nInd, uint8_t* SAnew, uint64_t nSAnewByte, float* ms) {
+    return star_gpu_addref_merge_sa((star_addref_t*)h, ind, nInd, SAnew, nSAnewByte, ms);
+}
+static void vt_addref_close(void* h) { star_gpu_addref_close((star_addref_t*)h); }
 static const star_engine_vtbl_t g_cuda_engine = {vt_init, vt_map, vt_destroy, star_gpu_last_error, vt_sjdb_open, vt_sjdb_search, vt_sjdb_merge, vt_sjdb_close, star_gpu_sa_build, vt_set_sj_novel,
                                                  star_gpu_host_alloc, star_gpu_host_free, vt_download, vt_signal_open, vt_signal_segment, vt_signal_close,
-                                                 vt_dedup_open, vt_dedup_batch, vt_dedup_close};
+                                                 vt_dedup_open, vt_dedup_batch, vt_dedup_close, vt_addref_open, vt_addref_search, vt_addref_merge, vt_addref_close};
 
 int star_cli_main(int argc, char** argv) { return star_cli_main_engine(argc, argv, &g_cuda_engine); }
 

@@ -119,7 +119,7 @@ int star_gpu_sjdb_merge_sa(star_sjdb_t* h, const uint64_t* indSorted, uint64_t n
     const u64 tiles = ((nSAnew + 63) / 64 + 31) / 32, want = (tiles + 3) / 4;   // 4 warps per CTA, one tile of 32 x 64 rows per warp and step
     const unsigned grid = (unsigned)(want < (u64)h->nSM * 8 ? (want ? want : 1) : (u64)h->nSM * 8);
     const size_t smemBytes = (size_t)4 * 32 * h->ix.saBits * 8;
-    SJ_CK(cudaFuncSetAttribute(sjdb_merge_sa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
+    SJ_CK(cudaFuncSetAttribute(sjdb_merge_sa_kernel<SjdbMerge>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
     sjdb_merge_sa_kernel<<<grid, 128, smemBytes>>>(h->ix, m, dOut);
     countLaunches(1);
     SJ_CK(cudaGetLastError());

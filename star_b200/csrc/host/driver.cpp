@@ -21,6 +21,7 @@
 #include <memory>
 #include <mutex>
 #include <random>
+#include <sstream>
 #include <thread>
 
 #include "host.h"
@@ -648,6 +649,10 @@ static int runAlign(int argc, char** argv, const star_engine_vtbl_t* eng) {
     rc = loadIndex(P.genomeDir, &P.hp, idx, err, &glog);
     logMain << glog << std::flush;
     if (rc) return exitWithError(err, rc, &logMain);
+    // ---- references added at the mapping stage (Genome_genomeLoad.cpp:374): before any junction insertion, so that the junctions and the
+    // GTF may name them; a 2-pass run maps both passes against the grown index
+    rc = addReferences(P, &P.hp, idx, eng, logMain, err);
+    if (rc) return exitWithError(err, rc, &logMain);
 
     // ---- on-the-fly junction insertion (STAR.cpp:145-150) and the 1st pass of --twopassMode Basic (twoPassRunPass1.cpp:9-96)
     SjdbLoci sjdbLoci;
@@ -827,6 +832,11 @@ static int mergeShards(int argc, char** argv, int nShards, const uint64_t* count
     LoadedIndex idx;
     rc = loadIndex(P.genomeDir, &P.hp, idx, err, nullptr, true);
     if (rc) { std::cerr << err << std::endl; return rc; }
+    {   // the references every shard added: names and lengths only
+        std::ostringstream addLog;
+        rc = addReferences(P, &P.hp, idx, nullptr, addLog, err, true);
+        if (rc) { std::cerr << err << std::endl; return rc; }
+    }
     OutputWriter W(P, idx);
     Stats total;
     std::vector<Junction> allSJ;
@@ -926,6 +936,11 @@ static int mergePass1(int argc, char** argv, int nShards, const char* dir) {
     LoadedIndex idx;
     rc = loadIndex(P.genomeDir, &P.hp, idx, err, nullptr, true);
     if (rc) { std::cerr << err << std::endl; return rc; }
+    {   // the references every shard added: names and lengths only
+        std::ostringstream addLog;
+        rc = addReferences(P, &P.hp, idx, nullptr, addLog, err, true);
+        if (rc) { std::cerr << err << std::endl; return rc; }
+    }
     P.outSAMtype = {"None"};
     OutputWriter W(P, idx);
     Stats total;

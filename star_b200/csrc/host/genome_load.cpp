@@ -5,9 +5,11 @@
 // (Genome_genomeLoad.cpp:471-520).  Shared-memory loading is not built: GPU HBM residency replaces it.
 #include <sys/stat.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <fstream>
+#include <ostream>
 #include <sstream>
 
 #include "host.h"
@@ -176,21 +178,7 @@ int loadIndex(const std::string& gDirIn, star_params_t* p, LoadedIndex& L, std::
             L.chrBin[ii] = ichr - 1;
         }
     }
-    // ---- window geometry :382-410
-    if (p->alignIntronMax == 0 && p->alignMatesGapMax == 0) {
-    } else {
-        p->winBinNbits = (uint64_t)std::floor(std::log2((double)(std::max(std::max(4ULL, (unsigned long long)p->alignIntronMax),
-                                                                          (p->alignMatesGapMax == 0 ? 1000ULL : (unsigned long long)p->alignMatesGapMax)) / 4)) + 0.5);
-        p->winBinNbits = std::max((uint64_t)p->winBinNbits, (uint64_t)std::floor(std::log2((double)(nGenome / 40000 + 1)) + 0.5));
-    }
-    if (p->winBinNbits > gChrBinNbits) p->winBinNbits = gChrBinNbits;
-    if (p->alignIntronMax == 0 && p->alignMatesGapMax == 0) {
-    } else {
-        p->winFlankNbins = std::max(p->alignIntronMax, p->alignMatesGapMax) / (1ULL << p->winBinNbits) + 1;
-        p->winAnchorDistNbins = 2 * p->winFlankNbins;
-    }
-    p->winBinChrNbits = gChrBinNbits - p->winBinNbits;
-    p->winBinN = nGenome / (1ULL << p->winBinNbits) + 1;
+    windowGeometry(p, nGenome, gChrBinNbits);
 
     v.nGenome = nGenome;
     v.nSA = nSA; v.nSAbyte = nSAbyte;
@@ -200,6 +188,25 @@ int loadIndex(const std::string& gDirIn, star_params_t* p, LoadedIndex& L, std::
     L.pointView();
     if (log) *log = lg.str();
     return 0;
+}
+
+// Genome_genomeLoad.cpp:382-410; recomputed from scratch on every call (after references are added, with the grown genome)
+void windowGeometry(star_params_t* p, uint64_t nGenome, uint32_t gChrBinNbits, std::ostream* logMain) {
+    if (p->alignIntronMax == 0 && p->alignMatesGapMax == 0) {
+    } else {
+        p->winBinNbits = (uint64_t)std::floor(std::log2((double)(std::max(std::max(4ULL, (unsigned long long)p->alignIntronMax),
+                                                                          (p->alignMatesGapMax == 0 ? 1000ULL : (unsigned long long)p->alignMatesGapMax)) / 4)) + 0.5);
+        p->winBinNbits = std::max((uint64_t)p->winBinNbits, (uint64_t)std::floor(std::log2((double)(nGenome / 40000 + 1)) + 0.5));
+        if (logMain) *logMain << "To accommodate alignIntronMax=" << p->alignIntronMax << " redefined winBinNbits=" << p->winBinNbits << "\n";
+    }
+    if (p->winBinNbits > gChrBinNbits) p->winBinNbits = gChrBinNbits;
+    if (p->alignIntronMax == 0 && p->alignMatesGapMax == 0) {
+    } else {
+        p->winFlankNbins = std::max(p->alignIntronMax, p->alignMatesGapMax) / (1ULL << p->winBinNbits) + 1;
+        p->winAnchorDistNbins = 2 * p->winFlankNbins;
+    }
+    p->winBinChrNbits = gChrBinNbits - p->winBinNbits;
+    p->winBinN = nGenome / (1ULL << p->winBinNbits) + 1;
 }
 
 void LoadedIndex::pointView() {

@@ -107,7 +107,9 @@ struct HostParams {
     std::string outMultimapperOrder = "Old_2.4";
     unsigned readNmates = 1;
     // --runMode genomeGenerate (Parameters.cpp:230-256)
-    std::vector<std::string> genomeFastaFiles = {"-"};
+    std::vector<std::string> genomeFastaFiles = {"-"};   // with --runMode alignReads: references added to the loaded index (addref.cpp)
+    std::vector<std::string> outSAMfilter = {"None"};    // KeepOnlyAddedReferences / KeepAllAddedReferences (ReadAlign_outputAlignments.cpp:140-164)
+    bool outSAMfilterKeepOnly = false, outSAMfilterKeepAll = false;
     uint64_t genomeSAindexNbases = 14, genomeChrBinNbits = 18, genomeSAsparseD = 1, limitGenomeGenerateRAM = 31000000000ULL;
     // on-the-fly junction insertion / 2-pass (Parameters.cpp:240-269, 779-825, 1000-1035)
     std::vector<std::string> sjdbFileChrStartEnd = {"-"};
@@ -159,6 +161,7 @@ struct LoadedIndex {
     bool sjdbInfoExists = false;
     std::string sjdbInsertSaveGenome;     // sjdbInsertSave of genomeParameters.txt ("" = index older than on-the-fly insertion)
     std::string genomeDir;
+    uint32_t insertChrFirst = ~0u;        // first chromosome added at the mapping stage (genomeInsertChrIndFirst; ~0: none added)
     void pointView();                     // re-points view.* at the vectors (after they were replaced)
 };
 
@@ -178,6 +181,20 @@ int genomeGenerate(HostParams& P, const star_engine_vtbl_t* eng, std::ostream& l
 int sjdbInsertJunctions(const HostParams& P, star_params_t* hp, LoadedIndex& idx, SjdbLoci& loci, bool pass2, const std::string& pass1sjFile,
                         const star_engine_vtbl_t* eng, std::ostream& logMain, std::string& err, bool generateMode = false);
 int loadIndex(const std::string& genomeDir, star_params_t* p, LoadedIndex& L, std::string& err, std::string* log, bool chrInfoOnly = false);
+// the index-dependent window geometry (Genome_genomeLoad.cpp:382-410): winBinNbits, winFlankNbins, winAnchorDistNbins, winBinChrNbits, winBinN
+void windowGeometry(star_params_t* p, uint64_t nGenome, uint32_t gChrBinNbits, std::ostream* logMain = nullptr);
+// genomeScanFastaFiles.cpp:5-91 (genome_generate.cpp): appends the chromosomes of `files` behind the ones in the (closed) lists, codes into
+// G[pad + position] when G is given.  Returns 0 or STAR_EXIT_INPUT_FILES with the message in err.
+int scanFastaFiles(const std::vector<std::string>& files, uint64_t binN, std::vector<std::string>& chrName, std::vector<uint64_t>& chrStart,
+                   std::vector<uint64_t>& chrLength, std::vector<uint8_t>* G, size_t pad, std::ostream& logMain, std::string& err);
+// genomeSAindex.cpp:6-220 over a whole suffix array (genome_generate.cpp)
+int buildSAindex(const uint8_t* G, uint64_t nGenome, const uint8_t* SA, uint64_t nSA, uint32_t GstrandBit, uint32_t Lmax, int runThreadN,
+                 std::vector<uint64_t>& genomeSAindexStart, std::vector<uint8_t>& SAistore, uint64_t& nSAi, uint64_t& nSAibyte, std::string& err);
+// --genomeFastaFiles at the mapping stage (addref.cpp; Genome_insertSequences.cpp, insertSeqSA.cpp): adds the sequences to the loaded index
+// before any junction insertion (device part through eng->addref_*), then re-runs windowGeometry.  chrInfoOnly: an index loaded with
+// loadIndex(..., chrInfoOnly) gets the added chromosomes' names, starts and lengths only.  Returns 0 or a STAR_EXIT_* code with the message in err.
+int addReferences(const HostParams& P, star_params_t* hp, LoadedIndex& idx, const star_engine_vtbl_t* eng, std::ostream& logMain, std::string& err,
+                  bool chrInfoOnly = false);
 
 // ---- signal tracks (signal.cpp; signalFromBAM.cpp:5-209): <prefix>Signal.{Unique,UniqueMultiple}.str{1,2}.out.{bg,wig} ----------------
 // recs: the BAM records in file order, each pointing at its block_size field; names / lens: the references of the header.

@@ -688,6 +688,8 @@ void OutputWriter::formatReads(const ReadChunk& c, const star_align_batch_t& out
         }
     };
     std::string scratch;
+    std::vector<star_align_t> keptTr;   // --outSAMfilter KeepAllAddedReferences: the alignments written
+    star_align_t bestCopy;
     for (uint32_t i = lo; i < hi; i++) {
         const star_read_result_t& r = out.reads[i];
         uint64_t L0 = c.lenTrue(i, 0);   // readLength after clipping (ReadAlign_oneRead.cpp: statsRA.readBases)
@@ -732,6 +734,33 @@ void OutputWriter::formatReads(const ReadChunk& c, const star_align_batch_t& out
                 for (uint64_t k = 0; k < nTr; k++) recordSJ(trs[k], nTr, sj, sjReadStartN);
             }
             // writeSAM :133-230
+            const star_align_t* trsAll = trs;
+            const star_align_t* bestP = &trsAll[r.bestTr];
+            if (P.outSAMfilterKeepOnly || P.outSAMfilterKeepAll) {   // --outSAMfilter :140-164, after the counters, junctions and quantifications
+                if (P.outSAMfilterKeepOnly) {   // an alignment on an old reference: nothing at all is written (unmapType stays < 0)
+                    bool old = false;
+                    for (uint64_t k = 0; k < nTr; k++) old = old || trs[k].Chr < idx.insertChrFirst;
+                    if (old) continue;
+                } else {   // only the alignments on added references; the first of them is primary; NH / HI / MAPQ count these
+                    keptTr.clear();
+                    int64_t bestKept = -1;
+                    for (uint64_t k = 0; k < nTr; k++)
+                        if (trs[k].Chr >= idx.insertChrFirst) {
+                            if (k == r.bestTr) bestKept = (int64_t)keptTr.size();
+                            keptTr.push_back(trs[k]);
+                            keptTr.back().primaryFlag = 0;
+                        }
+                    if (keptTr.empty()) continue;
+                    keptTr[0].primaryFlag = 1;
+                    // the best alignment (whose mates decide the unmapped-mate record) is not filtered, but it is the same object as its copy in
+                    // the list, so it carries the primary flag the filter gave that copy
+                    bestCopy = trsAll[r.bestTr];
+                    if (bestKept >= 0) bestCopy.primaryFlag = keptTr[bestKept].primaryFlag;
+                    bestP = &bestCopy;
+                    trs = keptTr.data();
+                    nTr = keptTr.size();
+                }
+            }
             bool mateMapped[2] = {false, false};
             uint64_t nWrite = std::min<uint64_t>(P.hp.outSAMmultNmax, nTr);
             for (uint64_t k = 0; k < nWrite; k++) {
@@ -750,7 +779,7 @@ void OutputWriter::formatReads(const ReadChunk& c, const star_align_batch_t& out
                     if (P.outBAMunsorted && P.unmappedKeepPairs && c.nMates > 1 && (!mm1[0] || !mm1[1])) bamUnmapped(c, i, r, &trs[k], 4, mm1, sam);   // (unsorted stream only)
                 }
             }
-            const star_align_t& best = trs[r.bestTr];
+            const star_align_t& best = *bestP;
             mateMapped[best.exFrag[0]] = true;
             mateMapped[best.exFrag[best.nExons - 1]] = true;
             if (c.nMates > 1 && !(mateMapped[0] && mateMapped[1])) unmapType = 4;

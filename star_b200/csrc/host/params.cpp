@@ -116,7 +116,7 @@ bool parseU64(const std::string& s, uint64_t& out) {
 // STAR parameters that exist in the reference but belong to subsystems outside the hot path (SURVEY.md §2)
 const char* kUnsupported[] = {
     "genomeChainFiles", "genomeFileSizes", "genomeTransformOutput", "genomeChrSetMitochondrial", "genomeSuffixLengthMax",
-    "genomeTransformType", "genomeTransformVCF", "genomeType", "varVCFfile", "readFilesType", "readFilesSAMattrKeep", "outSAMfilter",
+    "genomeTransformType", "genomeTransformVCF", "genomeType", "varVCFfile", "readFilesType", "readFilesSAMattrKeep",
     "peOverlapNbasesMin", "peOverlapMMp", "chimOutType",
     "chimSegmentMin", "chimScoreMin", "chimScoreDropMax", "chimScoreSeparation", "chimScoreJunctionNonGTAG", "chimJunctionOverhangMin",
     "chimSegmentReadGapMax", "chimFilter", "chimMainSegmentMultNmax", "chimMultimapNmax", "chimMultimapScoreRange",
@@ -185,7 +185,7 @@ int parseCommandLine(int argc, char** argv, HostParams& P, std::string& err) {
     STR("sjdbGTFfile", &P.sjdbGTFfile); STR("sjdbGTFchrPrefix", &P.sjdbGTFchrPrefix); STR("sjdbGTFfeatureExon", &P.sjdbGTFfeatureExon);
     STR("sjdbGTFtagExonParentTranscript", &P.sjdbGTFtagExonParentTranscript); STR("sjdbGTFtagExonParentGene", &P.sjdbGTFtagExonParentGene);
     VSTR("sjdbGTFtagExonParentGeneName", &P.sjdbGTFtagExonParentGeneName); VSTR("sjdbGTFtagExonParentGeneType", &P.sjdbGTFtagExonParentGeneType);
-    VSTR("genomeFastaFiles", &P.genomeFastaFiles); U64("genomeSAindexNbases", &P.genomeSAindexNbases); U64("genomeChrBinNbits", &P.genomeChrBinNbits);
+    VSTR("genomeFastaFiles", &P.genomeFastaFiles); VSTR("outSAMfilter", &P.outSAMfilter); U64("genomeSAindexNbases", &P.genomeSAindexNbases); U64("genomeChrBinNbits", &P.genomeChrBinNbits);
     U64("genomeSAsparseD", &P.genomeSAsparseD); U64("limitGenomeGenerateRAM", &P.limitGenomeGenerateRAM);
     VSTR("sjdbFileChrStartEnd", &P.sjdbFileChrStartEnd); U64("sjdbOverhang", &P.sjdbOverhang); STR("sjdbInsertSave", &P.sjdbInsertSave);
     U64("limitSjdbInsertNsj", &P.limitSjdbInsertNsj); STR("twopassMode", &P.twopassMode); U64("twopass1readsN", &P.twopass1readsN);
@@ -341,6 +341,13 @@ int finalizeParams(HostParams& P, std::string& err) {
     if (P.outWigNorm[0] == "None") P.wigNorm = 0;
     else if (P.outWigNorm[0] == "RPM") P.wigNorm = 1;
     else return bad("EXITING because of fatal parameter ERROR: unrecognized option in --outWigNorm=" + P.outWigNorm[0] + "\nSOLUTION: use one of the allowed values of --outWigNorm : 'None' or 'RPM' \n");
+    // Parameters.cpp:740-760 (the message names only two of the three values)
+    if (P.outSAMfilter[0] == "KeepOnlyAddedReferences") P.outSAMfilterKeepOnly = true;
+    else if (P.outSAMfilter[0] == "KeepAllAddedReferences") P.outSAMfilterKeepAll = true;
+    else if (P.outSAMfilter[0] != "None")
+        return bad("EXITING because of FATAL INPUT ERROR: unknown/unimplemented value for --outSAMfilter: " + P.outSAMfilter[0] + "\nSOLUTION: specify one of the allowed values: KeepOnlyAddedReferences or None\n");
+    if ((P.outSAMfilterKeepOnly || P.outSAMfilterKeepAll) && P.genomeFastaFiles[0] == "-")
+        return bad("EXITING because of FATAL INPUT ERROR: --outSAMfilter KeepOnlyAddedReferences OR KeepAllAddedReferences options can only be used if references are added on-the-fly with --genomeFastaFiles\nSOLUTION: use default --outSAMfilter None, OR add references with --genomeFataFiles\n");
     if (P.runMode == "inputAlignmentsFromBAM") {   // Parameters.cpp:566-607: no genome, no reads
         if (P.bamRemoveDuplicatesType == "UniqueIdentical") { P.dedupYes = true; P.dedupMarkMulti = true; }
         else if (P.bamRemoveDuplicatesType == "UniqueIdenticalNotMulti") { P.dedupYes = true; P.dedupMarkMulti = false; }
@@ -366,6 +373,9 @@ int finalizeParams(HostParams& P, std::string& err) {
     if (P.genomeLoad == "LoadAndKeep" || P.genomeLoad == "LoadAndRemove") {   // the index lives in this process' HBM; nothing is shared or kept
         if (P.twopassMode != "None" || P.sjdbFileChrStartEnd[0] != "-" || P.sjdbGTFfile != "-")   // Parameters.cpp:809-814, 1012-1017
             return bad("EXITING because of fatal PARAMETERS error: on the fly junction insertion and 2-pass mappng cannot be used with shared memory genome \nSOLUTION: run STAR with --genomeLoad NoSharedMemory to avoid using shared memory\n");
+        // the reference does not size the insert on its shared-memory path (Genome_genomeLoad.cpp:245-250 is the NoSharedMemory branch only)
+        if (P.genomeFastaFiles[0] != "-")
+            return bad("EXITING because of fatal PARAMETERS error: references cannot be added with --genomeFastaFiles to a shared memory genome (--genomeLoad " + P.genomeLoad + ")\nSOLUTION: run STAR with --genomeLoad NoSharedMemory to add references at the mapping stage\n");
         P.genomeLoad = "NoSharedMemory";
     }
     if (P.genomeLoad != "NoSharedMemory")

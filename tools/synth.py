@@ -232,6 +232,24 @@ def make_annotation(chrs, preset, seed=3):
     return trs
 
 
+def make_spikes(chrs, n=92, seed=92, copy_len=20000):
+    """References to add at the mapping stage: n ERCC-like spikes of 400-2000 random bases (a third end in the same 30-base poly-A tail) and
+    a copy of copy_len bases of the first chromosome.  Returns list of (name, uint8 ASCII array), the copy last."""
+    rng = np.random.default_rng(seed)
+    out = []
+    for i in range(n):
+        s = ACGT[rng.integers(0, 4, size=int(rng.integers(400, 2001)), dtype=np.uint8)]
+        if i % 3 == 0:
+            s[-30:] = ord("A")
+        out.append(("ERCC-%05d" % (i + 1), s))
+    seq = chrs[0][1]
+    p = int(rng.integers(0, len(seq) - copy_len))
+    while np.any(seq[p:p + copy_len] == ord("N")):
+        p = int(rng.integers(0, len(seq) - copy_len))
+    out.append(("copy_%s_%d" % (chrs[0][0], p + 1), seq[p:p + copy_len].copy()))
+    return out
+
+
 def write_fasta(chrs, path):
     with open(path, "wb") as f:
         for name, seq in chrs:
